@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """bench.py -- 10 ms frames/sec of the batched denoise hot path (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams S] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams S] [--impl b200|reference] [--dump-outputs DIR]
   (N > 1: launched by torchrun, one rank per GPU; streams shard with no collective -> "weak")
 
 One "step" = one call of the hot path = one 480-sample frame for each of S streams resident on a
@@ -12,6 +12,8 @@ GPU (default S = 4096 = BASELINE configs[1], default synthetic model).  Prints O
   roofline   dominant kernel: algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json
   cpu_baseline  the unmodified reference (oracle/_ref, AVX2 RTCD build) on this box's host cores
 --impl reference times that CPU reference arm alone on the same workload.
+--dump-outputs DIR writes what the last timed step computed (denoised PCM and VAD of every stream, see dump_outputs)
+so that two builds can be compared output for output: the inputs depend only on the arguments.
 """
 import argparse
 import json
@@ -41,6 +43,24 @@ KERNEL_BYTES = {
     "k_net": 1292 + 2688 + 3 * 6144,
     "k_heads": 6276,
 }
+
+
+DUMP_LIMIT = 64 << 20   # bytes written by --dump-outputs at most
+
+
+def dump_outputs(d, out, vad):
+    """out [S][480], vad [S] (float32) of the last timed step -> d/pcm.npy, d/vad.npy.  Past DUMP_LIMIT bytes a fixed,
+    seeded sample of the streams is written instead, their indices in d/stream_index.npy."""
+    os.makedirs(d, exist_ok=True)
+    S = out.shape[0]
+    # per kept stream: 480 PCM + 1 VAD float32 + the float64 index; 4 KB for the three .npy headers
+    keep = (DUMP_LIMIT - 4096) // ((FRAME + 1) * 4 + 8)
+    if S > keep:
+        idx = np.sort(np.random.default_rng(0).choice(S, keep, replace=False))
+        out, vad = out[idx], vad[idx]
+        np.save(os.path.join(d, "stream_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(d, "pcm.npy"), np.ascontiguousarray(out, np.float32))
+    np.save(os.path.join(d, "vad.npy"), np.ascontiguousarray(vad, np.float32))
 
 
 def world():
@@ -247,6 +267,8 @@ def single_process(a, cfg, S, K, Wm):
     wall_ms = (time.perf_counter() - t0) * 1e3
     ms = max(e0.elapsed_time(e1) for e0, e1 in ev)
     clocks = sampler.stop()
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, torch.cat([o.cpu() for o in out_d]).numpy(), torch.cat([v.cpu() for v in vad_d]).numpy())
     batch.process_device_multi([o.data_ptr() for o in out_d], [p[(Wm + K) % F].data_ptr() for p in pool_d], [v.data_ptr() for v in vad_d])
     batch.sync()
     value = G * S * K / (ms * 1e-3)
@@ -288,6 +310,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--model", default="default", help="model name under tests/golden/models (default, little, ...) or a blob path")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     ap.add_argument("--single-process", action="store_true",
                     help="with --gpus N and no torchrun: ONE process drives N GPUs through rnnoise_batch_create_multi (C ABI sharding)")
     a = ap.parse_args()
@@ -299,7 +322,7 @@ def main():
     cfg = {"workload": f"{S} concurrent 48 kHz mono streams per GPU, {a.model} synthetic model (int8 block-sparse GRUs), "
                        f"one 480-sample frame per stream per step", "streams_per_gpu": S, "frame": FRAME,
            "model": os.path.relpath(MODEL, ROOT),
-           "l2": f"per-step state+I/O working set {S * 43344 / 1e6:.0f} MB vs 126 MB L2; input rotates through a "
+           "l2": f"per-step state+I/O working set {S * 43344 / 1e6:.0f} MB vs 50 MB L2; input rotates through a "
                  f"{pool_frames(S)}-frame device pool ({pool_frames(S) * S * FRAME * 4 / 1e6:.0f} MB)"}
 
     if a.impl == "reference":
@@ -311,7 +334,7 @@ def main():
         # CPU work in total (the rate does not depend on how many frames are run)
         ref = reference_baseline(total_S, 60.0, model=MODEL, warmup=min(Wm, 5))
         if ref is None:
-            print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/ref_bench not built (needs /root/reference at build time)"}))
+            print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/ref_bench not built (needs the reference sources at build time)"}))
             return
         v = ref["frames_per_s"]
         print(json.dumps({"impl": "reference", "metric": "10ms frames/sec", "value": v, "unit": "frames/s", "n_gpus": a.gpus,
@@ -380,6 +403,15 @@ def main():
     wall_ms = (time.perf_counter() - t_wall) * 1e3
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop()
+    if a.dump_outputs:
+        # the whole job's output: with several ranks every shard is gathered (rank r holds streams r*S .. r*S + S - 1)
+        outs, vads = [out_d], [vad_d]
+        if W > 1:
+            outs, vads = [torch.empty_like(out_d) for _ in range(W)], [torch.empty_like(vad_d) for _ in range(W)]
+            dist.all_gather(outs, out_d)
+            dist.all_gather(vads, vad_d)
+        if rank == 0:
+            dump_outputs(a.dump_outputs, torch.cat(outs).cpu().numpy(), torch.cat(vads).cpu().numpy())
     # one prefilter hint is still pending (frame Wm+K): consume it so the host-call path starts clean
     batch.process_device(out_d.data_ptr(), pool_d[(Wm + K) % POOL_FRAMES].data_ptr(), vad_d.data_ptr())
     batch.sync()
@@ -457,22 +489,14 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
-    traffic = None
-    try:   # dram__bytes_read+write per launch of that kernel from the committed ncu --set full capture
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        key = "k_gru" if top.startswith("k_gru") else top
-        if S == 4096 and key in tj and tj.get("lanes", 1) == lanes and a.model == "default":
-            traffic = tj[key]["dram_bytes_per_launch"]
-    except Exception:
-        pass
+    hbm = peaks.get("hbm_gbs", 3350.0)
     top_bytes = KERNEL_BYTES.get(top, 43344) * S // lanes           # one launch covers one lane's streams
     ms_launch = kernels[top] / lanes
     achieved = top_bytes / (ms_launch * 1e-3) / 1e9
     roof = {"kernel": top, "bound": "hbm", "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "fallback 6650 GB/s",
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s",
             "algorithmic_bytes_per_launch": top_bytes, "ms_per_launch": ms_launch, "launches_per_step": lanes,
-            "streams_per_launch": S // lanes, "traffic": traffic,
+            "streams_per_launch": S // lanes,
             "kernel_ms_per_step": kernels, "kernel_share": {k: v / sum(kernels.values()) for k, v in kernels.items()},
             "pipeline": {"algorithmic_bytes_per_stream_frame": 43344,
                          "achieved_GBps": 43344 * S * K / (ms * 1e-3) / 1e9 / 1.0,

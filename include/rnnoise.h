@@ -1,7 +1,7 @@
-/* rnnoise.h -- public C ABI of the B200-native batched denoise engine (librnnoise_b200.so).
+/* rnnoise.h -- public C ABI of the H100-native batched denoise engine (librnnoise_b200.so).
  *
  * Drop-in surface of xiph/rnnoise's include/rnnoise.h (reference file:line cited per entry point)
- * plus the batched entry points the B200 engine adds.  Plain C linkage, plain pointers and sizes,
+ * plus the batched entry points the GPU engine adds.  Plain C linkage, plain pointers and sizes,
  * no CUDA or torch types in any signature.  Every entry point that computes runs on the GPU; there
  * is no CPU fallback: creation fails (NULL / -1) when no CUDA device is usable.
  *
@@ -116,8 +116,8 @@ RNNOISE_EXPORT void rnnoise_batch_destroy(RNNoiseBatch *b);
 RNNOISE_EXPORT int rnnoise_batch_get_streams(const RNNoiseBatch *b);
 /** Inside a device batch the DSP stages of a frame (analysis front, output tail) run as 1..4 "lanes" -- sub-grids over
  *  contiguous stream ranges on their own CUDA streams -- while the network runs once over the whole batch; streams are
- *  independent, so results do not depend on the split.  The default (two lanes from 1024 up to 32767 streams, else one;
- *  measured on B200) can be overridden with $RNNOISE_B200_LANES at creation time.  Returns the number of lanes. */
+ *  independent, so results do not depend on the split.  The default (two lanes from 1024 up to 32767 streams, else one)
+ *  can be overridden with $RNNOISE_B200_LANES at creation time.  Returns the number of lanes. */
 RNNOISE_EXPORT int rnnoise_batch_get_lanes(const RNNoiseBatch *b);
 
 /** Host-buffer call: in/out are [nb_streams][480] floats in host memory (pinned memory makes the

@@ -1,6 +1,6 @@
 """rnnoise_b200 -- host-side mirror of the C ABI in include/rnnoise.h (ctypes, no compute in Python).
 
-The product is rnnoise_b200/librnnoise_b200.so (C host code + sm_100a CUDA kernels).  This module
+The product is rnnoise_b200/librnnoise_b200.so (C host code + sm_90a CUDA kernels).  This module
 only loads it and forwards calls with plain pointers, the way the reference's own callers
 (examples/rnnoise_demo.c:40-66) use librnnoise.  It never falls back to a CPU path: importing works
 without a GPU (so the ABI can be inspected), but creating a batch raises if the engine cannot come up.

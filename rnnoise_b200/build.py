@@ -1,6 +1,6 @@
-"""Builds rnnoise_b200/librnnoise_b200.so in-tree: host C (gcc) + CUDA for sm_100a (nvcc).
+"""Builds rnnoise_b200/librnnoise_b200.so in-tree: host C (gcc) + CUDA for sm_90a (nvcc).
 
-  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo --fmad=false ...
+  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo --fmad=false ...
 --fmad=false is part of the arithmetic contract (DESIGN.md "Numerics"): the reference's DSP code is
 compiled without FMA contraction; every FMA the kernels execute is an explicit fmaf().
 """
@@ -16,7 +16,7 @@ SO = os.path.join(HERE, "librnnoise_b200.so")
 # through $RNNOISE_B200_LIB_PATH to measure what the contract costs and what contraction does to pitch parity.
 SO_FMAD = os.path.join(HERE, "librnnoise_b200_fmad.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _newer(target, deps):

@@ -1,4 +1,4 @@
-// dsp_core.cuh -- per-stream DSP stages of rnnoise_process_frame() for the B200 engine.
+// dsp_core.cuh -- per-stream DSP stages of rnnoise_process_frame() for the GPU engine.
 //
 // One CTA of DSP_THREADS threads owns one stream for one frame; every stage below is written as
 // a barrier-separated PHASE so that (a) on the GPU the 4 warps cooperate through shared memory and
@@ -198,7 +198,7 @@ HD cpx csub(cpx a, cpx b) { cpx m; m.r = a.r - b.r; m.i = a.i - b.i; return m; }
 // a permutation of each aligned block of 16 that moves the four 4-element groups of block B by B mod 4 places.  The
 // second stage (radix 4, m = 4) reads elements 16 g + j + 4 q with (g, j) = lane: unswizzled, the 16 lanes of a half
 // warp hit only 4 of the 16 8-byte bank pairs (a 4-way conflict on all 8 accesses of a butterfly: 3x the wavefronts
-// of that stage, a quarter of all shared-memory wavefronts of the spectrum and synthesis kernels, profiles/r2p);
+// of that stage, a quarter of all shared-memory wavefronts of the spectrum and synthesis kernels);
 // swizzled, bank = j + 4 (q ^ (g & 3)) takes all 16 values.  The other stages walk j or u linearly inside a block
 // (the XOR is then a constant per half warp) and stay conflict-free; stage 1 still writes 4 contiguous elements.
 // Arithmetic and results are untouched: only where an element is parked between stages changes.

@@ -39,12 +39,8 @@ struct SpectrumArgs {
 // packed side by side into the lanes of one or two warps -- same instructions, PITCH_NS x the useful
 // lanes.  Thread ids: q = tid / PITCH_THREADS is the stream a thread belongs to, t its local id;
 // packed phases use the first lanes of the CTA instead.
-// Measured on B200 (S = 4096), kernel alone / whole pipelined step:
-//   128 threads per stream: PITCH_NS 1 -> 127 us / 403 us, PITCH_NS 4 -> 145 us (16 streams resident per
-//     SM either way: packing removes instructions but leaves fewer warps runnable during the chains)
-//    96 threads per stream: PITCH_NS 1 -> 132 us / 377-383 us (18 streams per SM: the 1 KB the hardware
-//     reserves per CTA costs two of the 20), PITCH_NS 2 -> 131 / 377, PITCH_NS 4 -> 124 us / 365 us
-//     (5 CTAs x 4 = 20 streams, the thread-slot limit) -> default.
+// 96 threads per stream and PITCH_NS 4: 5 CTAs x 4 = 20 streams resident per SM (the thread-slot limit; with one stream
+// per CTA the 1 KB the hardware reserves per CTA costs two of them).  128 threads per stream leave 16 streams per SM.
 #ifndef PITCH_NS
 #define PITCH_NS 4
 #endif
@@ -554,7 +550,7 @@ HD void spectrum_stream(float *sm, const SpectrumArgs a, const DspTables *T) {
       // difference.  32 dependent steps of 3 float ops instead of conversions and FP64 ops on one thread
       // (tests/test_dsp_emulation.py holds this source against the literal double form).
       // The chain runs on registers: 16 inputs per 16-byte vector loads, 16 steps, 16 outputs per vector stores (one
-      // shared-memory round trip per step made this phase 11 % of the CTA's lifetime, profiles/r2p).
+      // shared-memory round trip per step made this phase 11 % of the CTA's lifetime).
 #pragma unroll
       for (int hb = 0; hb < NB_BANDS; hb += 16) {
         f4 v[4];
@@ -683,8 +679,7 @@ struct SynthesisArgs {
 #define SS_F (SS_P + 2 * 400)         // [1920] FFT buffer
 #define SS_V (SS_F + 2 * WINDOW_SIZE) // [6][34] band vectors: r, norm, g, sums...
 #define SS_TOTAL (SS_V + 6 * 34)
-// 3886 floats: 14 CTAs per SM (13 with all 481 bins of P resident; measured r2j: 0.2900 -> 0.2875 ms per step at 4096
-// streams, 1.098 -> 1.095 at 16 384).  Prefetching the synthesis window next to the overlap memory would need 960
+// 3886 floats: 14 CTAs per SM (13 with all 481 bins of P resident).  Prefetching the synthesis window next to the overlap memory would need 960
 // floats there and cost that 14th CTA; the window is a table every CTA reads (L1 / L2 hits).
 static_assert((SS_TOTAL * 4 + 1024) * 14 <= 228 * 1024, "synthesis kernel: 14 CTAs per SM");
 
@@ -787,7 +782,7 @@ HD void synthesis_stream(float *sm, const SynthesisArgs a, const DspTables *T) {
   // P is dead once the pitch filter has run: fetch the overlap memory into its place with asynchronous copies now, and --
   // X being dead once stage 1 has gathered it -- the synthesis window into X's place during the next phase, so that the
   // output phase waits neither on HBM nor on the L2 for them (it was 30 % of this CTA's lifetime: four dependent
-  // round trips per thread for the window, profiles/r2p)
+  // round trips per thread for the window)
   float *ola = sm + SS_P + 2;   // 16-byte aligned
   float *hws = sm + SS_X;
   PHASE_BEGIN

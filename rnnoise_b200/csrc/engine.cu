@@ -1,4 +1,4 @@
-// engine.cu -- device arena, model upload and the per-frame kernel sequence of the B200 engine.
+// engine.cu -- device arena, model upload and the per-frame kernel sequence of the GPU engine.
 //
 // One frame of every stream =
 //   k_biquad (thread/stream) -> k_pitch, k_spectrum (CTA/stream) -> k_conv1 -> conv2 -> GRU x3 -> k_heads
@@ -174,8 +174,7 @@ __global__ void __launch_bounds__(PG_THREADS, PG <= 8 ? 2 : 1) k_pitch2(Arena a,
 }
 
 // 12 CTAs per SM = 40 registers per thread without spills.  The shared-memory plan would admit 14, but 32 registers
-// spill in the radix-5 stage and the pipelined step gets slower (r2j: 0.2900 -> 0.2965 ms at 4096 streams, 1.098 ->
-// 1.123 at 16 384) although a range's grid then is a single wave.
+// spill in the radix-5 stage.
 #ifndef SPEC_MIN_BLOCKS
 #define SPEC_MIN_BLOCKS 12
 #endif
@@ -564,14 +563,12 @@ extern "C" B200Engine *b200_engine_create_on(const B200HostModel *m, int S, int 
   e->ev_in = nullptr;
   const char *ov = getenv("RNNOISE_B200_OVERLAP");
   e->overlap = !(ov && !strcmp(ov, "0"));
-  // measured on B200 (S = 4096): early-launched dependents hold smem/thread slots the overlapping analysis
-  // kernels could use: 10.05 M frames/s without vs 9.0-9.3 M with PDL -> opt-in only
+  // programmatic dependent launch is opt-in: early-launched dependents hold smem/thread slots the overlapping analysis
+  // kernels could use
   { const char *pd = getenv("RNNOISE_B200_PDL"); e->pdl = pd && !strcmp(pd, "1"); }
   {
-    // Ranges of the DSP stages (measured on B200, profiles/r2f_ab_matrix.json, ms per step with 1 / 2 / 3 ranges:
-    // 1024 streams 0.113 / 0.113 / 0.195, 2048: 0.190 / 0.177-0.186 / 0.243, 4096: 0.320-0.330 / 0.305 / 0.352,
-    // 8192: 0.606 / 0.593 / 0.622, 16384: 1.144 / 1.136 / 1.153): two from 1024 to 32767 streams, else one; whole
-    // 128-stream tiles except the last.  $RNNOISE_B200_LANES overrides.
+    // Ranges of the DSP stages: two from 1024 to 32767 streams, else one (kernels of about one wave overlap with each
+    // other and with the other stages); whole 128-stream tiles except the last.  $RNNOISE_B200_LANES overrides.
     const char *ln = getenv("RNNOISE_B200_LANES");
     int nr = ln && atoi(ln) > 0 ? atoi(ln) : (S >= 1024 && S < 32768) ? 2 : 1;
     if (nr > B200_MAX_RANGES) nr = B200_MAX_RANGES;
@@ -585,7 +582,7 @@ extern "C" B200Engine *b200_engine_create_on(const B200HostModel *m, int S, int 
     }
     // stream priorities: the tails (oldest frame) and the network first, the analysis fronts last -- the front of frame
     // f+1 only fills what the back of frame f leaves free.  (Capping the front kernels' grid to leave room was measured
-    // and is worse than the plain one-CTA-per-stream grid: profiles/README.md.)
+    // to be worse than the plain one-CTA-per-stream grid.)
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);   // lo = lowest priority (largest value)
     const char *pr = getenv("RNNOISE_B200_FRONT_PRIORITY");
@@ -630,16 +627,16 @@ extern "C" B200Engine *b200_engine_create_on(const B200HostModel *m, int S, int 
     ok = upload_q(e, &dm.gru_in[k], &m->gru_in[k]) == 0 && upload_q(e, &dm.gru_rec[k], &m->gru_rec[k]) == 0 &&
          m->gru_rec[k].diag && upload_gru_params(e, &dm.gru_rec[k], &m->gru_in[k], &m->gru_rec[k], m->gru) == 0;
   // tensor-core GRU path: permuted weights + TMA maps for both frame parities
-  // RNNOISE_B200_GRU_KERNEL = tc2 (default: persistent pipelined tcgen05) | tc1 (one tile per CTA) |
+  // RNNOISE_B200_GRU_KERNEL = tc2 (default: persistent pipelined wgmma) | tc1 (one tile per CTA) |
   // dp4a (CUDA-core cross-check); all three produce identical bits
   { const char *hk = getenv("RNNOISE_B200_HEADS_KERNEL"); e->heads2 = !(hk && !strcmp(hk, "cpasync")); }
   // Pitch kernel: v1 (4 streams x 96 threads per CTA, 20 streams resident per SM) is the default; v2 (k_pitch2, 16
   // streams per CTA, far fewer instructions but one CTA per SM) has the same throughput per SM and only wins when a
-  // lane is exactly one wave of its CTAs (profiles/README.md "Pitch kernels"); $RNNOISE_B200_PITCH_KERNEL = v1 | v2.
+  // lane is exactly one wave of its CTAs; $RNNOISE_B200_PITCH_KERNEL = v1 | v2.
   { const char *pk = getenv("RNNOISE_B200_PITCH_KERNEL"); e->pitch2 = pk && !strcmp(pk, "v2"); }
   ok = ok && cudaFuncSetAttribute(k_pitch2, cudaFuncAttributeMaxDynamicSharedMemorySize, PITCH2_SMEM_BYTES) == cudaSuccess;
   // streams per CTA of the heads kernel: 16 while the batch is small (twice the CTAs: lower latency), 32 once the GPU is
-  // full (fewer, fatter CTAs disturb the other stages less: 4096 streams 0.3008 vs 0.3055 ms per step; 8: 0.3245)
+  // full (fewer, fatter CTAs disturb the other stages less)
   { const char *ht = getenv("RNNOISE_B200_HEADS_TILE"); e->heads_ns = ht ? (!strcmp(ht, "32w") ? 8 : !strcmp(ht, "32") ? 4 : !strcmp(ht, "8") ? 1 : 2) : device_streams >= 4096 ? 4 : 2; }
   ok = ok && cudaFuncSetAttribute(k_heads2<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, h2_smem_bytes<1>()) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(k_heads2<4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, h2_smem_bytes<4>()) == cudaSuccess;
@@ -675,10 +672,10 @@ extern "C" B200Engine *b200_engine_create_on(const B200HostModel *m, int S, int 
     e->conv_maps.h = e->conv_maps.x; e->conv_maps.wr = e->conv_maps.wi;
     ok = ok && cudaFuncSetAttribute(k_tc2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2_smem_bytes<false>(a.Kcp, m->gru)) == cudaSuccess;
   }
-  // fused network kernel (net_kernel.cuh): needs the persistent tcgen05 GRU path and conv2 on the tensor cores
+  // fused network kernel (net_kernel.cuh): needs the persistent wgmma GRU path and conv2 on the tensor cores
   // The fused kernel removes five launches and their drain/fill gaps per frame: it wins while the batch is latency-bound
-  // (S = 64: 0.064 vs 0.080 ms per frame) and loses once the GPU is full, where its CTAs idle through the cluster barriers
-  // on SMs nothing else can share (S = 4096: 0.34 vs 0.32 ms): default up to 512 streams per device.
+  // and loses once the GPU is full, where its CTAs idle through the cluster barriers on SMs nothing else can share:
+  // default up to 512 streams per device.
   // $RNNOISE_B200_NET_KERNEL = fused | layers overrides.
   {
     const char *nk = getenv("RNNOISE_B200_NET_KERNEL");
@@ -687,9 +684,7 @@ extern "C" B200Engine *b200_engine_create_on(const B200HostModel *m, int S, int 
   }
   {
     // CTAs per cluster of k_net.  8 halves every CTA's share of a layer (and the kernel's latency) but takes twice
-    // the SMs per 128-stream tile (measured on B200, network time per frame: S = 64: 59 vs 88 us, S = 1024: 125 vs
-    // 187 us; S = 2048: step 0.206 vs 0.195 ms; S = 4096: 268 vs 213 us): default 8 up to 8 tiles (1024 streams) on the
-    // device.  $RNNOISE_B200_NET_CLUSTER = 4 | 8 overrides.
+    // the SMs per 128-stream tile: default 8 up to 8 tiles (1024 streams) on the device.  $RNNOISE_B200_NET_CLUSTER = 4 | 8 overrides.
     const char *nc = getenv("RNNOISE_B200_NET_CLUSTER");
     const int tiles = (device_streams + TC_M - 1) / TC_M;
     int want = nc ? atoi(nc) : tiles <= 8 ? 8 : 4;

@@ -1,19 +1,15 @@
-// gru_tc.cuh -- one GRU layer for 128 streams x 32 hidden units per CTA on the 5th-gen tensor cores.
+// gru_tc.cuh -- the int8 tensor-core kernels of the network on Hopper (wgmma): one GRU layer or conv2 per launch.
 //
-//   D_in [128 x 96] = Xu8[128 x K] . Wi_slice^T      (u8 x s8 -> s32, tcgen05.mma kind::i8)
-//   D_rec[128 x 96] = Hu8[128 x K] . Wr_slice^T      96 = {z, r, n} x 32 units, K = gru (384)
+//   D_in [M x 3U] = Xu8[M x K] . Wi_slice^T      (u8 x s8 -> s32, wgmma.mma_async m64nNk32)
+//   D_rec[M x 3U] = Hu8[M x K] . Wr_slice^T      3U = {z, r, n} x U units, K = gru (384)
 //
-// Operands arrive by TMA (cp.async.bulk.tensor, SWIZZLE_128B, K-major) straight from the u8 mirrors
-// of the activations / the pre-permuted s8 weights; both accumulators live in TMEM (192 of 256
-// allocated columns); one elected thread issues the 2 x (K/32) MMAs and commits to an mbarrier;
-// the four epilogue warps read their TMEM lane quarter with tcgen05.ld and apply, in registers,
-// exactly the arithmetic of the reference (compute_linear + compute_generic_gru, src/nnet_arch.h:
-// 130-162, src/nnet.c:65-94): (float)acc*scale + subias, fma(diag,h,.), sigmoid/sigmoid/tanh,
-// h' = z*h + (1-z)*n, then store h' as fp32 AND as the u8 operand of the next consumer.
-// The integer accumulators are exact, so this kernel is bit-identical to the dp4a kernel k_gru.
-//
-// grid = (ceil(S/128), gru/32), block = 160 (warps 0..3 epilogue, warp 4 = TMA + MMA issuer),
-// dynamic smem = GRU_TC_SMEM bytes, 1 CTA / SM.
+// Operands arrive by TMA (cp.async.bulk.tensor, SWIZZLE_128B, K-major) straight from the u8 mirrors of the
+// activations / the pre-permuted s8 weights, and wgmma reads them through shared-memory matrix descriptors.  The s32
+// accumulators live in the registers of the warpgroup that issued the MMAs; that warpgroup applies, in registers,
+// exactly the arithmetic of the reference (compute_linear + compute_generic_gru, src/nnet_arch.h:130-162,
+// src/nnet.c:65-94): (float)acc*scale + subias, fma(diag,h,.), sigmoid/sigmoid/tanh, h' = z*h + (1-z)*n, then stores
+// h' as fp32 AND as the u8 operand of the next consumer.  The integer accumulators are exact, so these kernels are
+// bit-identical to the dp4a kernels k_gru / k_conv2.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -21,11 +17,11 @@
 
 #include "rnn_kernels.cuh"
 
-#define TC_M 128          // streams per CTA (UMMA M)
-#define TC_UNITS 32       // hidden units per CTA
-#define TC_N (3 * TC_UNITS)  // UMMA N = 96
+#define TC_M 128          // streams per CTA tile: two 64-row wgmma halves
+#define TC_UNITS 32       // hidden units per CTA of k_gru_tc
+#define TC_N (3 * TC_UNITS)  // wgmma N of k_gru_tc = 96
 #define TC_KATOM 128      // bytes of K per 128B-swizzle atom
-#define TC_TMEM_COLS 256  // power of two >= 2 * TC_N
+#define TC_HALF_BYTES (64 * TC_KATOM)   // byte offset of rows 64..127 inside an A atom
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -34,6 +30,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -60,51 +59,178 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 B apart
-// (cute::UMMA::SmemDescriptor: start>>4 | LBO(=1)<<16 | SBO(1024>>4)<<32 | version 1 <<46 | SW128(2)<<61)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+
+// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 B apart (wgmma matrix descriptor:
+// start>>4 | LBO(unused by this layout, 1)<<16 | SBO(1024>>4)<<32 | SWIZZLE_128B(1)<<62).  The tile base is
+// 1024-byte aligned, so the descriptor's base offset is 0; +2 in the start field advances K by 32 bytes.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// cute::UMMA::InstrDescriptor for kind::i8: D = S32, A = U8, B = S8, both K-major
-__device__ __forceinline__ uint32_t umma_idesc_i8(int M, int N) {
-  return (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// after wgmma_wait_all(): keeps every use of the accumulators behind the wait
+template <int R>
+__device__ __forceinline__ void wgmma_hold(int (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 32 B] . B[N x 32 B]^T, u8 x s8 -> s32; acc = 0 overwrites D
+__device__ __forceinline__ void wgmma_i8(int (&d)[8], uint64_t a, uint64_t b, int acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+      : "l"(a), "l"(b), "r"(acc)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, int (&v)[16]) {
+__device__ __forceinline__ void wgmma_i8(int (&d)[24], uint64_t a, uint64_t b, int acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+        "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
+      : "l"(a), "l"(b), "r"(acc)
       : "memory");
+}
+__device__ __forceinline__ void wgmma_i8(int (&d)[48], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
+      "%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+        "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]),
+        "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+// d = A[64 rows x K] . B[N rows x K]^T over `natoms` 128-byte K atoms (A atoms a_stride, B atoms b_stride bytes apart),
+// issued by the whole warpgroup; the caller fences before and commits / waits after
+// wgmma_chain unrolls the chain for its atom count (1..8, K <= 1024): with a run-time loop ptxas serialises the wgmma of
+// the chain and inserts warpgroup fences of its own (C7515 / C7520 in `build.py -v`).  k_net keeps the run-time loop
+// (wgmma_chain_rt): a 544-thread CTA gets at most 96 registers per thread, and the unrolled chains of its four layer
+// shapes raise its spills from ~0.3 KB to ~1 KB of loads per thread.
+template <int NA, int R>
+__device__ __forceinline__ void wgmma_chain_n(int (&d)[R], uint32_t A, int a_stride, uint32_t B, int b_stride) {
+#pragma unroll
+  for (int a = 0; a < NA; a++) {
+    const uint64_t ad = wgmma_desc_sw128(A + a * a_stride), bd = wgmma_desc_sw128(B + a * b_stride);
+#pragma unroll
+    for (int k = 0; k < TC_KATOM / 32; k++) wgmma_i8(d, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (a | k) ? 1 : 0);
+  }
+}
+template <int R>
+__device__ __forceinline__ void wgmma_chain_rt(int (&d)[R], uint32_t A, int a_stride, uint32_t B, int b_stride, int natoms) {
+  for (int a = 0; a < natoms; a++) {
+    const uint64_t ad = wgmma_desc_sw128(A + a * a_stride), bd = wgmma_desc_sw128(B + a * b_stride);
+#pragma unroll
+    for (int k = 0; k < TC_KATOM / 32; k++) wgmma_i8(d, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (a | k) ? 1 : 0);
+  }
+}
+template <int R>
+__device__ __forceinline__ void wgmma_chain(int (&d)[R], uint32_t A, int a_stride, uint32_t B, int b_stride, int natoms) {
+  switch (natoms) {
+    case 1: wgmma_chain_n<1>(d, A, a_stride, B, b_stride); break;
+    case 2: wgmma_chain_n<2>(d, A, a_stride, B, b_stride); break;
+    case 3: wgmma_chain_n<3>(d, A, a_stride, B, b_stride); break;
+    case 4: wgmma_chain_n<4>(d, A, a_stride, B, b_stride); break;
+    case 5: wgmma_chain_n<5>(d, A, a_stride, B, b_stride); break;
+    case 6: wgmma_chain_n<6>(d, A, a_stride, B, b_stride); break;
+    case 7: wgmma_chain_n<7>(d, A, a_stride, B, b_stride); break;
+    default: wgmma_chain_n<8>(d, A, a_stride, B, b_stride); break;
+  }
+}
+
+// Accumulator fragment of wgmma m64nNk32 (PTX ISA, "Register fragments", matrix D): thread `lane` of warp w of the
+// warpgroup holds d[4 j + 2 h + e] = D[16 (w % 4) + lane / 4 + 8 h][8 j + 2 (lane % 4) + e] for every 8-column block j.
+// Of a block of U units per gate (the N columns are z | r | n, U each) a thread therefore owns the rows
+// 16 (w % 4) + lane / 4 + {0, 8} and, in each, the P = U / 4 units frag_unit(q): neighbour pairs 8 i + 2 (lane % 4) + {0, 1}.
+__device__ __forceinline__ int frag_unit(int q) { return 8 * (q >> 1) + 2 * (int)(threadIdx.x & 3) + (q & 1); }
+template <int U>
+__device__ __forceinline__ int frag_idx(int g, int h, int q) { return 4 * ((U / 8) * g + (q >> 1)) + 2 * h + (q & 1); }
+__device__ __forceinline__ int frag_row(int warp) { return 16 * (warp & 3) + ((int)(threadIdx.x & 31) >> 2); }
+
+// fp32 values of a thread's P units of one row (row -> unit 0 of the tile; pairs of neighbours: 8-byte loads)
+template <int P>
+__device__ __forceinline__ void frag_load_row(const float *row, float (&v)[P]) {
+#pragma unroll
+  for (int k = 0; k < P / 2; k++) {
+    const float2 t = __ldg((const float2 *)&row[frag_unit(2 * k)]);
+    v[2 * k] = t.x; v[2 * k + 1] = t.y;
+  }
+}
+// the fp32 outputs and their u8 operand mirror
+template <int P>
+__device__ __forceinline__ void frag_store_row(float *row, uint8_t *row_u8, const float (&v)[P]) {
+#pragma unroll
+  for (int k = 0; k < P / 2; k++) {
+    const int u = frag_unit(2 * k);
+    *(float2 *)&row[u] = make_float2(v[2 * k], v[2 * k + 1]);
+    *(uint16_t *)&row_u8[u] = (uint16_t)(quant_u8(v[2 * k]) | (quant_u8(v[2 * k + 1]) << 8));
+  }
+}
+// GRU update of row h (0 / 1) of a thread's fragment of a U-unit tile from the input (ai) and recurrent (ar)
+// accumulators; prm = the tile's epilogue parameter records [U][16] (DevLayerQ::packed): {sc_i, sb_i, sc_r, sb_r} for
+// z, r, n, then {diag_z, diag_r, diag_n, 0}
+template <int U>
+__device__ __forceinline__ void gru_frag(const int (&ai)[3 * U / 2], const int (&ar)[3 * U / 2], const float *prm, int h,
+                                         const float (&hold)[U / 4], float (&out)[U / 4]) {
+  constexpr int P = U / 4;
+  float zi[P], ri[P], ni[P], zr[P], rr[P], nr[P];
+#pragma unroll
+  for (int q = 0; q < P; q++) {
+    const float *pu = prm + 16 * frag_unit(q);
+    const float x = hold[q];
+    const float4 pz = *(const float4 *)&pu[0], pr = *(const float4 *)&pu[4];
+    const float4 pn = *(const float4 *)&pu[8], pd = *(const float4 *)&pu[12];
+    zi[q] = (float)ai[frag_idx<U>(0, h, q)] * pz.x + pz.y;
+    ri[q] = (float)ai[frag_idx<U>(1, h, q)] * pr.x + pr.y;
+    ni[q] = (float)ai[frag_idx<U>(2, h, q)] * pn.x + pn.y;
+    zr[q] = fmaf(pd.x, x, (float)ar[frag_idx<U>(0, h, q)] * pz.z + pz.w);
+    rr[q] = fmaf(pd.y, x, (float)ar[frag_idx<U>(1, h, q)] * pr.z + pr.w);
+    nr[q] = fmaf(pd.z, x, (float)ar[frag_idx<U>(2, h, q)] * pn.z + pn.w);
+  }
+  gru_units<P>(zi, ri, ni, zr, rr, nr, hold, out);
+}
+// conv2 output (tanh(acc * scale + subias)) of row h of a thread's fragment of a 16-unit slice; scale / subias -> unit 0
+__device__ __forceinline__ void conv_frag(const int (&acc)[8], const float *scale, const float *subias, int h, float (&out)[4]) {
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    const int u = frag_unit(q);
+    out[q] = (float)acc[frag_idx<16>(0, h, q)] * scale[u] + subias[u];
+  }
+  if (fabsf(out[0]) < ACT_FAST_LIMIT && fabsf(out[1]) < ACT_FAST_LIMIT && fabsf(out[2]) < ACT_FAST_LIMIT && fabsf(out[3]) < ACT_FAST_LIMIT) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) out[q] = act_tanh_inrange(out[q]);
+  } else {
+#pragma unroll
+    for (int q = 0; q < 4; q++) out[q] = act_tanh(out[q]);
+  }
 }
 
 struct GruTcMaps {
-  CUtensorMap x, h, wi, wr;   // x,h: u8 [S][K]; wi,wr: s8 [(K/32 slices) * 96][K] permuted
+  CUtensorMap x, h, wi, wr;   // x,h: u8 [S][K]; wi,wr: s8 [(K/units slices) * 3 * units][K] permuted
 };
 
-// smem: A tiles (X, H): 2 x (K/128) x 16 KB ; B tiles (Wi, Wr): 2 x (K/128) x 12 KB ; params ; barriers
+// ================================================================================================
+// k_gru_tc -- one GRU layer, one tile of 128 streams x 32 units per CTA (cross-check of k_tc2).
+// grid = (ceil(S/128), gru/32), block = 160: warps 0..3 = the warpgroup that issues the MMAs (M64 x N96 per matrix,
+// the two 64-row halves of the tile in turn) and runs the epilogue; warp 4 = TMA producer.
+// dynamic smem = gru_tc_smem_bytes(gru), 1 CTA / SM.
+// ================================================================================================
+// smem: A tiles (X, H): 2 x (K/128) x 16 KB ; B tiles (Wi, Wr): 2 x (K/128) x 12 KB ; parameters ; barrier
 #define TC_A_ATOM_BYTES (TC_M * TC_KATOM)     // 16384
 #define TC_B_ATOM_BYTES (TC_N * TC_KATOM)     // 12288
 __host__ __device__ constexpr int gru_tc_smem_bytes(int gru) {
-  return 1024 /*align slack*/ + 2 * (gru / TC_KATOM) * (TC_A_ATOM_BYTES + TC_B_ATOM_BYTES) + 15 * TC_UNITS * 4 + 64;
+  return 1024 /*align slack*/ + 2 * (gru / TC_KATOM) * (TC_A_ATOM_BYTES + TC_B_ATOM_BYTES) + 16 * TC_UNITS * 4 + 64;
 }
 
 __global__ void __launch_bounds__(160, 1)
 k_gru_tc(int S, int gru, const __grid_constant__ GruTcMaps maps, DevLayerQ wi, DevLayerQ wr,
          const float *__restrict__ h_old, float *__restrict__ h_new, uint8_t *__restrict__ h_new_u8,
          const int *__restrict__ silence) {
+  (void)wi;   // its epilogue parameters are part of the layer's packed records (wr.packed)
   extern __shared__ uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.x * TC_M, j0 = blockIdx.y * TC_UNITS, natoms = gru / TC_KATOM;
@@ -113,30 +239,18 @@ k_gru_tc(int S, int gru, const __grid_constant__ GruTcMaps maps, DevLayerQ wi, D
   uint8_t *base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t *sAx = base, *sAh = sAx + natoms * TC_A_ATOM_BYTES;
   uint8_t *sBi = sAh + natoms * TC_A_ATOM_BYTES, *sBr = sBi + natoms * TC_B_ATOM_BYTES;
-  float *prm = (float *)(sBr + natoms * TC_B_ATOM_BYTES);       // [15][32]
-  uint64_t *bars = (uint64_t *)(prm + 15 * TC_UNITS);           // [0] operands landed, [1] MMAs done
-  uint32_t *tmem_slot = (uint32_t *)(bars + 2);
-  const uint32_t bar_full = smem_u32(&bars[0]), bar_mma = smem_u32(&bars[1]);
+  float *prm = (float *)(sBr + natoms * TC_B_ATOM_BYTES);       // [32][16]: packed records of the tile's units
+  uint64_t *bars = (uint64_t *)(prm + 16 * TC_UNITS);           // [0] operands landed
+  const uint32_t bar_full = smem_u32(&bars[0]);
 
   if (tid == 0) {
     mbar_init(bar_full, 1);
-    mbar_init(bar_mma, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {   // TMEM allocation is warp-wide; the same warp frees it at the end
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TC_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // epilogue parameters of this unit slice: [g] scale_i, subias_i, scale_r, subias_r, diag
-  for (int i = tid; i < 15 * TC_UNITS; i += blockDim.x) {
-    int which = i / (3 * TC_UNITS), g = (i / TC_UNITS) % 3, u = i % TC_UNITS;
-    const float *src = which == 0 ? wi.scale : which == 1 ? wi.subias : which == 2 ? wr.scale : which == 3 ? wr.subias : wr.diag;
-    prm[i] = src[g * gru + j0 + u];
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  if (warp < 4)
+    for (int c = tid; c < 4 * TC_UNITS; c += 128) cp_async16(prm + 4 * c, wr.packed + (size_t)j0 * 16 + 4 * c, true);
+  asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
 
   if (warp == 4) {
     if (lane == 0) {
@@ -150,86 +264,45 @@ k_gru_tc(int S, int gru, const __grid_constant__ GruTcMaps maps, DevLayerQ wi, D
         tma_load_2d(smem_u32(sAh + a * TC_A_ATOM_BYTES), &maps.h, bar_full, a * TC_KATOM, m0);
         tma_load_2d(smem_u32(sBr + a * TC_B_ATOM_BYTES), &maps.wr, bar_full, a * TC_KATOM, blockIdx.y * TC_N);
       }
-      // ---- MMA issuer ----
-      mbar_wait(bar_full, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t idesc = umma_idesc_i8(TC_M, TC_N);
-      for (int g = 0; g < 2; g++) {
-        const uint8_t *A = g ? sAh : sAx, *B = g ? sBr : sBi;
-        for (int a = 0; a < natoms; a++) {
-          const uint64_t ad = umma_desc_sw128(smem_u32(A + a * TC_A_ATOM_BYTES));
-          const uint64_t bd = umma_desc_sw128(smem_u32(B + a * TC_B_ATOM_BYTES));
-#pragma unroll
-          for (int k = 0; k < TC_KATOM / 32; k++)   // UMMA K = 32 bytes; advance inside the swizzle atom
-            umma_i8(tmem + g * TC_N, ad + (uint64_t)(k * 32 >> 4), bd + (uint64_t)(k * 32 >> 4), idesc, (a | k) ? 1u : 0u);
-        }
-      }
-      umma_commit(bar_mma);   // implies tcgen05.fence::before_thread_sync
     }
-  } else {
-    // ---- epilogue warps: thread = stream row (TMEM lane 32*warp + lane) ----
-    const int s = m0 + warp * 32 + lane;
-    const bool live = s < S;
-    const bool silent = live ? silence[s] != 0 : true;
-    float hrow[TC_UNITS];
-    if (live) {
-#pragma unroll
-      for (int q = 0; q < TC_UNITS / 4; q++) {
-        float4 v = *(const float4 *)&h_old[(size_t)s * gru + j0 + 4 * q];
-        hrow[4 * q] = v.x; hrow[4 * q + 1] = v.y; hrow[4 * q + 2] = v.z; hrow[4 * q + 3] = v.w;
-      }
-    } else {
-#pragma unroll
-      for (int q = 0; q < TC_UNITS; q++) hrow[q] = 0.f;
-    }
-    mbar_wait(bar_mma, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
-#pragma unroll
-    for (int half = 0; half < 2; half++) {
-      int az[16], ar[16], an[16], bz[16], br[16], bn[16];
-      const int c = half * 16;
-      tmem_ld16(trow + 0 * TC_UNITS + c, az); tmem_ld16(trow + 1 * TC_UNITS + c, ar); tmem_ld16(trow + 2 * TC_UNITS + c, an);
-      tmem_ld16(trow + TC_N + 0 * TC_UNITS + c, bz); tmem_ld16(trow + TC_N + 1 * TC_UNITS + c, br); tmem_ld16(trow + TC_N + 2 * TC_UNITS + c, bn);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      float outv[16];
-#pragma unroll
-      for (int q = 0; q < 16; q++) {
-        const int u = c + q;
-        const float h = hrow[u];
-        float out = h;
-        if (!silent) {
-          float zi = (float)az[q] * prm[(0 * 3 + 0) * TC_UNITS + u] + prm[(1 * 3 + 0) * TC_UNITS + u];
-          float ri = (float)ar[q] * prm[(0 * 3 + 1) * TC_UNITS + u] + prm[(1 * 3 + 1) * TC_UNITS + u];
-          float ni = (float)an[q] * prm[(0 * 3 + 2) * TC_UNITS + u] + prm[(1 * 3 + 2) * TC_UNITS + u];
-          float zr = fmaf(prm[(4 * 3 + 0) * TC_UNITS + u], h, (float)bz[q] * prm[(2 * 3 + 0) * TC_UNITS + u] + prm[(3 * 3 + 0) * TC_UNITS + u]);
-          float rr = fmaf(prm[(4 * 3 + 1) * TC_UNITS + u], h, (float)br[q] * prm[(2 * 3 + 1) * TC_UNITS + u] + prm[(3 * 3 + 1) * TC_UNITS + u]);
-          float nr = fmaf(prm[(4 * 3 + 2) * TC_UNITS + u], h, (float)bn[q] * prm[(2 * 3 + 2) * TC_UNITS + u] + prm[(3 * 3 + 2) * TC_UNITS + u]);
-          float z = act_sigmoid(zi + zr);
-          float r = act_sigmoid(ri + rr);
-          float n = act_tanh(ni + nr * r);
-          out = z * h + (1 - z) * n;
-        }
-        outv[q] = out;
-      }
-      if (live) {
-        float *dst = &h_new[(size_t)s * gru + j0 + c];
-#pragma unroll
-        for (int q = 0; q < 4; q++) *(float4 *)&dst[4 * q] = make_float4(outv[4 * q], outv[4 * q + 1], outv[4 * q + 2], outv[4 * q + 3]);
-        uint4 pk;
-        pk.x = quant4(outv[0], outv[1], outv[2], outv[3]);
-        pk.y = quant4(outv[4], outv[5], outv[6], outv[7]);
-        pk.z = quant4(outv[8], outv[9], outv[10], outv[11]);
-        pk.w = quant4(outv[12], outv[13], outv[14], outv[15]);
-        *(uint4 *)&h_new_u8[(size_t)s * gru + j0 + c] = pk;
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TC_TMEM_COLS) : "memory");
+  mbar_wait(bar_full, 0);
+  for (int mh = 0; mh < 2; mh++) {
+    const int r0 = m0 + 64 * mh + frag_row(warp);
+    bool live[2], silent[2];
+    float hold[2][TC_UNITS / 4];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int row = r0 + 8 * h;
+      live[h] = row < S;
+      silent[h] = live[h] ? silence[row] != 0 : true;
+      if (live[h]) frag_load_row(h_old + (size_t)row * gru + j0, hold[h]);
+      else
+#pragma unroll
+        for (int q = 0; q < TC_UNITS / 4; q++) hold[h][q] = 0.f;
+    }
+    int ai[3 * TC_UNITS / 2], ar[3 * TC_UNITS / 2];
+#pragma unroll
+    for (int i = 0; i < 3 * TC_UNITS / 2; i++) ai[i] = ar[i] = 0;
+    wgmma_fence();
+    wgmma_chain(ai, smem_u32(sAx) + mh * TC_HALF_BYTES, TC_A_ATOM_BYTES, smem_u32(sBi), TC_B_ATOM_BYTES, natoms);
+    wgmma_chain(ar, smem_u32(sAh) + mh * TC_HALF_BYTES, TC_A_ATOM_BYTES, smem_u32(sBr), TC_B_ATOM_BYTES, natoms);
+    wgmma_commit();
+    wgmma_wait_all();
+    wgmma_hold(ai); wgmma_hold(ar);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      float outv[TC_UNITS / 4];
+      if (silent[h]) {
+#pragma unroll
+        for (int q = 0; q < TC_UNITS / 4; q++) outv[q] = hold[h][q];
+      } else {
+        gru_frag<TC_UNITS>(ai, ar, prm, h, hold[h], outv);
+      }
+      const size_t row = (size_t)(r0 + 8 * h);
+      if (live[h]) frag_store_row(h_new + row * gru + j0, h_new_u8 + row * gru + j0, outv);
+    }
   }
 }
 
@@ -238,48 +311,47 @@ k_gru_tc(int S, int gru, const __grid_constant__ GruTcMaps maps, DevLayerQ wi, D
 //
 //   kGru = true : one GRU layer (k_gru_tc2).   kGru = false: conv2 (k_conv2_tc), a single GEMM + tanh.
 //
-// CTA = 128 streams x (N/4) output units, processed as slices of 16 units through a two-deep TMA ring
-// (TC2_STAGES) for the weight slices and a two-deep TMEM ring for the accumulators:
-//     warp 16 (one elected thread): TMA producer + tcgen05.mma issuer
-//     warps 0..15 (512 threads)   : epilogue -- warp w reads TMEM lane quarter (w & 3), units 4*(w>>2)..+4
-// so that  TMA / MMA(slice s+1) || epilogue(slice s).  The u8 activation tiles (128 x K;
-// GRU: Xu8 and Hu8) are loaded once per CTA and stay resident.  Per slice and matrix one
-// tcgen05.mma.kind::i8 chain of K/32 instructions, M128 x N48 (GRU: z|r|n of 16 units) or N16 (conv2);
-// accumulators: GRU [in z|r|n (48) | rec z|r|n (48)] = 96 TMEM columns per stage, conv2 16.
+// CTA = 128 streams x (N/4) output units, processed as slices of 16 units; the weight slices stream through a
+// TC2_STAGES-deep TMA ring (see ring_stage below):
+//     warp 16 (one elected thread): TMA producer
+//     warps 0..15 = four warpgroups : warpgroup g takes rows 64 (g & 1) .. + 64 of the slices s with s % 2 == g >> 1,
+//                                     issues their MMAs and runs their epilogue
+// so that the MMAs of one slice run beside the epilogue of the other warpgroup pair's slice.  The u8 activation tiles
+// (128 x K; GRU: Xu8 and Hu8) are loaded once per CTA and stay resident.  Per slice and matrix one wgmma chain of
+// K/32 instructions, M64 x N48 (GRU: z|r|n of 16 units) or N16 (conv2), accumulators in registers.
 // Same arithmetic as the dp4a kernels k_gru / k_conv2: bit-identical results.
 // grid = (ceil(S/128), 4), block = 544, 1 CTA / SM.
 // ================================================================================================
 #define P_SLICE 16
+// Weight rings: job j (a slice) is consumed by warpgroup pair j & 1, and each pair owns half of the stages, which it
+// uses in turn.  So every load into a stage is consumed by the same pair, in the order the loads were issued, and the
+// phase parity a consumer waits for always names the load it wants: a stage shared by both pairs could be waited on
+// while the other pair's earlier load into it is still in flight (TMA completions are not ordered), and the wait would
+// pass on the stale phase.  Stage counts are therefore even.  A pair releases its stage when its MMAs have retired,
+// long before its epilogue ends, so one stage per pair keeps the producer ahead of the MMAs.
 #ifndef P_STAGES
-#define P_STAGES 3                        // weight ring of the fused network kernel (net_kernel.cuh)
+#define P_STAGES 2                        // weight ring of the fused network kernel (net_kernel.cuh)
 #endif
-// Weight ring of the per-layer kernels: TWO stages.  The epilogue of a slice (2.7 us) is far longer than a slice's TMA +
-// MMAs, so the third stage never ran ahead usefully, while its 37 KB are what lets three CTAs of the DSP kernels share
-// an SM with a GRU CTA (same-box A/B at 4096 streams, profiles/r2p: 0.2804 -> 0.2775 ms per step, twice).
 #ifndef TC2_STAGES
-#define TC2_STAGES 2
+#define TC2_STAGES 2                      // weight ring of the per-layer kernels
 #endif
-// How many slices ahead the epilogue fetches the old state (1 or 2).  Two slices ahead take a layer from 22.3 to 21.0 us
-// at 4096 streams but cost 8 registers per thread (94 instead of 86), which leaves room for one CTA less of the DSP
-// kernels beside a GRU CTA: the pipelined step is slower with it (0.2790 vs 0.2770 ms, profiles/r2q_ab_4096.txt).
-#ifndef TC2_HAHEAD
-#define TC2_HAHEAD 1
-#endif
+static_assert(P_STAGES % 2 == 0 && P_STAGES >= 2 && P_STAGES <= 4, "P_STAGES: 2 or 4 (one or two stages per warpgroup pair)");
+static_assert(TC2_STAGES % 2 == 0 && TC2_STAGES >= 2 && TC2_STAGES <= 4, "TC2_STAGES: 2 or 4 (one or two stages per warpgroup pair)");
+// stage of job j in a ring of `stages`, and how many earlier jobs used that stage (its phase count)
+__host__ __device__ constexpr int ring_stage(int j, int stages) { return (j & 1) * (stages / 2) + (j >> 1) % (stages / 2); }
+__host__ __device__ constexpr int ring_use(int j, int stages) { return (j >> 1) / (stages / 2); }
 // L2 prefetch of the CTA's old-state rows at kernel start (no registers held): the state was written a whole frame ago
-// and has left the L2 at large batch sizes, so the per-slice gathers of the epilogue otherwise wait on HBM.  Same-box
-// A/B at 4096 streams (profiles/r2t_ab_4096.txt): 0.2570 -> 0.2564 ms per step -- inside the noise, kept on because it
-// costs nothing; it is the build the r2t evidence was measured with.
+// and has left the L2 at large batch sizes, so the per-slice gathers of the epilogue otherwise wait on HBM.
 #ifndef TC2_H_L2PF
 #define TC2_H_L2PF 1
 #endif
-#define P_TMEM_COLS 256                   // >= 2 stages x 96 columns, power of two
 
 template <bool kGru> struct TcCfg {
   static constexpr int kMats = kGru ? 2 : 1;                 // GEMMs per slice (input, recurrent)
-  static constexpr int kN = kGru ? 3 * P_SLICE : P_SLICE;    // UMMA N: 48 / 16
+  static constexpr int kN = kGru ? 3 * P_SLICE : P_SLICE;    // wgmma N: 48 / 16
   static constexpr int kBAtom = kN * TC_KATOM;               // bytes of one weight atom: 6144 / 2048
   static constexpr int kPrm = kGru ? 16 : 2;                 // epilogue parameters per unit (GRU: 4 float4, see below)
-  static constexpr int kCols = kMats * kN;                   // TMEM columns per stage: 96 / 16
+  static constexpr int kAcc = kN / 2;                        // accumulator registers per thread and matrix: 24 / 8
 };
 template <bool kGru>
 __host__ __device__ constexpr int tc2_smem_bytes(int K, int N) {
@@ -287,18 +359,10 @@ __host__ __device__ constexpr int tc2_smem_bytes(int K, int N) {
          TC2_STAGES * TcCfg<kGru>::kMats * (K / TC_KATOM) * TcCfg<kGru>::kBAtom + TcCfg<kGru>::kPrm * (N / 4) * 4 + 16 * 8 + 64;
 }
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-#define P_EPI_WARPS 16                    // epilogue warps: 4 per TMEM lane quarter
-#define P_UPT (P_SLICE / (P_EPI_WARPS / 4))   // units per epilogue thread and slice: 4
+#define P_EPI_WARPS 16                    // MMA + epilogue warps: four warpgroups
+#define P_PAIR_WARPS 8                    // warps of the warpgroup pair that consumes one slice
+#define P_UPT (P_SLICE / 4)               // units per thread and row of a slice: 4
 #define P_THREADS (32 * (P_EPI_WARPS + 1))
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, int (&v)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-               : "r"(taddr)
-               : "memory");
-}
 
 // K = contraction length = bytes of one (zero-weight padded) activation row, a multiple of 128; N = number of output
 // units (gru, a multiple of 64); ldo = row stride of the u8 output mirror (the padded K of its consumer).
@@ -322,19 +386,13 @@ k_tc2(int S, int K, int N, int ldo, const __grid_constant__ GruTcMaps maps, DevL
   const int stage_bytes = C::kMats * natoms * C::kBAtom;
   float *prm = (float *)(sB + TC2_STAGES * stage_bytes);            // [kPrm][upc]
   uint64_t *bars = (uint64_t *)(prm + C::kPrm * upc);
-  uint32_t *tmem_slot = (uint32_t *)(bars + 16);
   const uint32_t bar_a = smem_u32(&bars[0]);
   auto bar_bfull = [&](int i) { return smem_u32(&bars[1 + i]); };
-  auto bar_bempty = [&](int i) { return smem_u32(&bars[4 + i]); };
-  auto bar_tfull = [&](int i) { return smem_u32(&bars[7 + i]); };
-  auto bar_tempty = [&](int i) { return smem_u32(&bars[9 + i]); };
+  auto bar_bempty = [&](int i) { return smem_u32(&bars[8 + i]); };
 
   pdl_trigger();
-  // The producer thread initialises the barriers ITSELF and starts the weight and operand-tile loads right away:
-  // they overlap the TMEM allocation and the (scattered) parameter staging below instead of following them (the
-  // other threads touch the barriers only after the __syncthreads that ends the prologue).
-  auto load_B0 = [&](int s) {
-    const int st = s % TC2_STAGES;
+  auto load_B = [&](int s) {
+    const int st = ring_stage(s, TC2_STAGES);
     uint8_t *dst = sB + st * stage_bytes;
     const int row = (blockIdx.y * nslice + s) * C::kN;
     mbar_expect_tx(bar_bfull(st), (uint32_t)stage_bytes);
@@ -343,31 +401,28 @@ k_tc2(int S, int K, int N, int ldo, const __grid_constant__ GruTcMaps maps, DevL
       if (kGru) tma_load_2d(smem_u32(dst + (natoms + a) * C::kBAtom), &maps.wr, bar_bfull(st), a * TC_KATOM, row);
     }
   };
+  // The producer thread initialises the barriers ITSELF and starts the weight and operand-tile loads right away:
+  // they overlap the (scattered) parameter staging below instead of following it (the other threads touch the
+  // barriers only after the __syncthreads that ends the prologue).
   if (warp == P_EPI_WARPS && lane == 0) {
     mbar_init(bar_a, 1);
-    for (int i = 0; i < TC2_STAGES; i++) { mbar_init(bar_bfull(i), 1); mbar_init(bar_bempty(i), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(bar_tfull(i), 1); mbar_init(bar_tempty(i), P_EPI_WARPS); }
+    for (int i = 0; i < TC2_STAGES; i++) { mbar_init(bar_bfull(i), 1); mbar_init(bar_bempty(i), P_PAIR_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    // first what the first slice needs (its weights, then the operand tiles), then the second weight stage: every CTA
-    // of the grid starts here at the same time and the burst is bound by L2 bandwidth (17 MB at 4096 streams)
-    load_B0(0);                                                    // weights: independent of the previous kernel
+    // first what the first slice needs (its weights, then the operand tiles), then the other weight stages: every CTA
+    // of the grid starts here at the same time and the burst is bound by L2 bandwidth
+    load_B(0);                                                     // weights: independent of the previous kernel
     pdl_wait();                                                    // activations of this frame are complete
     mbar_expect_tx(bar_a, (uint32_t)(C::kMats * natoms * TC_A_ATOM_BYTES));
     for (int a = 0; a < natoms; a++) {
       tma_load_2d(smem_u32(sAx + a * TC_A_ATOM_BYTES), &maps.x, bar_a, a * TC_KATOM, m0);
       if (kGru) tma_load_2d(smem_u32(sAh + a * TC_A_ATOM_BYTES), &maps.h, bar_a, a * TC_KATOM, m0);
     }
-    for (int s = 1; s < TC2_STAGES && s < nslice; s++) load_B0(s);
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    for (int s = 1; s < TC2_STAGES && s < nslice; s++) load_B(s);
   }
   if (kGru) {
     // per unit u: {sc_i, sb_i, sc_r, sb_r} for z, r, n, then {diag_z, diag_r, diag_n, 0} (four LDS.128 in the epilogue):
     // this CTA's slice of the layer's packed records (DevLayerQ::packed) is contiguous -- 16-byte asynchronous copies
-    // issued by the epilogue warps, which wait for them only right before their first slice (the three dependent
-    // scattered loads per thread of the earlier staging loop were 8-14 % of this kernel's warp time, profiles/r2p)
+    // issued by the MMA warps, which wait for them only right before their first slice
     const float *src = wr.packed + (size_t)jq * 16;
     if (warp < P_EPI_WARPS)
       for (int c = tid; c < 4 * upc; c += 32 * P_EPI_WARPS) cp_async16(prm + 4 * c, src + 4 * c, true);
@@ -375,140 +430,74 @@ k_tc2(int S, int K, int N, int ldo, const __grid_constant__ GruTcMaps maps, DevL
   } else {
     for (int i = tid; i < C::kPrm * upc; i += blockDim.x) prm[i] = (i < upc ? wi.scale : wi.subias)[jq + i % upc];
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
 
   if (warp == P_EPI_WARPS) {
-    if (lane == 0) {
-      auto load_B = [&](int s) {
-        const int st = s % TC2_STAGES;
-        uint8_t *dst = sB + st * stage_bytes;
-        const int row = (blockIdx.y * nslice + s) * C::kN;
-        mbar_expect_tx(bar_bfull(st), (uint32_t)stage_bytes);
-        for (int a = 0; a < natoms; a++) {
-          tma_load_2d(smem_u32(dst + a * C::kBAtom), &maps.wi, bar_bfull(st), a * TC_KATOM, row);
-          if (kGru) tma_load_2d(smem_u32(dst + (natoms + a) * C::kBAtom), &maps.wr, bar_bfull(st), a * TC_KATOM, row);
-        }
-      };
-      mbar_wait(bar_a, 0);   // (weights and operand tiles were requested in the prologue)
-      const uint32_t idesc = umma_idesc_i8(TC_M, C::kN);
-      for (int s = 0; s < nslice; s++) {
-        const int st = s % TC2_STAGES, ts = s & 1;
-        mbar_wait(bar_bfull(st), (uint32_t)((s / TC2_STAGES) & 1));
-        mbar_wait(bar_tempty(ts), (uint32_t)(((s >> 1) & 1) ^ 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint8_t *Bs = sB + st * stage_bytes;
-        for (int g = 0; g < C::kMats; g++) {
-          const uint8_t *A = g ? sAh : sAx;
-          for (int a = 0; a < natoms; a++) {
-            const uint64_t ad = umma_desc_sw128(smem_u32(A + a * TC_A_ATOM_BYTES));
-            const uint64_t bd = umma_desc_sw128(smem_u32(Bs + (g * natoms + a) * C::kBAtom));
-#pragma unroll
-            for (int k = 0; k < TC_KATOM / 32; k++)
-              umma_i8(tmem + ts * C::kCols + g * C::kN, ad + (uint64_t)(k * 32 >> 4), bd + (uint64_t)(k * 32 >> 4), idesc, (a | k) ? 1u : 0u);
-          }
-        }
-        umma_commit(bar_bempty(st));   // weight stage reusable once these MMAs retire
-        umma_commit(bar_tfull(ts));    // accumulators of slice s ready for the epilogue
-        if (s >= 1 && s - 1 + TC2_STAGES < nslice) {   // refill the stage slice s-1 used
-          mbar_wait(bar_bempty((s - 1) % TC2_STAGES), (uint32_t)(((s - 1) / TC2_STAGES) & 1));
-          load_B(s - 1 + TC2_STAGES);
-        }
+    if (lane == 0)
+      for (int s = TC2_STAGES; s < nslice; s++) {   // refill a stage once the pair that read it has released it
+        mbar_wait(bar_bempty(ring_stage(s, TC2_STAGES)), (uint32_t)((ring_use(s, TC2_STAGES) - 1) & 1));
+        load_B(s);
       }
-    }
-  } else {
-    const int lq = warp & 3, ch = warp >> 2;
-    const int srow = m0 + lq * 32 + lane;
-    const bool live = srow < S;
-    const bool silent = live ? silence[srow] != 0 : true;
-    const uint32_t trow = tmem + ((uint32_t)(lq * 32) << 16);
-    float hcur[P_UPT], hnext[P_UPT], hnext2[P_UPT];   // old state: fetched two slices ahead (a strided 16-byte gather from HBM)
-    auto load_h = [&](int s, float (&dst)[P_UPT]) {
-      if (kGru && live && s < nslice) {
-        float4 a = __ldg((const float4 *)&h_old[(size_t)srow * N + jq + s * P_SLICE + ch * P_UPT]);
-        dst[0] = a.x; dst[1] = a.y; dst[2] = a.z; dst[3] = a.w;
-      } else {
-#pragma unroll
-        for (int q = 0; q < P_UPT; q++) dst[q] = 0.f;
-      }
-    };
-    if (TC2_H_L2PF && kGru && live)   // the row's upc floats = upc / 32 lines of 128 bytes, one per column group of the warp quartet
-      for (int l = ch; l * 32 < upc; l += P_EPI_WARPS / 4)
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(&h_old[(size_t)srow * N + jq + l * 32]) : "memory");
-    load_h(0, hcur);
-    if (TC2_HAHEAD == 2) load_h(1, hnext);
-    if (kGru) {   // the parameter records requested in the prologue: own copies landed, then visible to all epilogue warps
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * P_EPI_WARPS) : "memory");
-    }
-    for (int s = 0; s < nslice; s++) {
-      const int ts = s & 1;
-      if (TC2_HAHEAD == 2) load_h(s + 2, hnext2); else load_h(s + 1, hnext);
-      mbar_wait(bar_tfull(ts), (uint32_t)((s >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t t0 = trow + ts * C::kCols + ch * P_UPT;
-      const int ub = s * P_SLICE + ch * P_UPT;     // unit index inside this CTA's quarter
-      float outv[P_UPT];
-      if (kGru) {
-        int az[P_UPT], ar[P_UPT], an[P_UPT], bz[P_UPT], br[P_UPT], bn[P_UPT];
-        tmem_ld4(t0 + 0 * P_SLICE, az); tmem_ld4(t0 + 1 * P_SLICE, ar); tmem_ld4(t0 + 2 * P_SLICE, an);
-        tmem_ld4(t0 + C::kN + 0 * P_SLICE, bz); tmem_ld4(t0 + C::kN + 1 * P_SLICE, br); tmem_ld4(t0 + C::kN + 2 * P_SLICE, bn);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        // accumulators are in registers: hand the TMEM stage back to the MMA issuer
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_tempty(ts));
-        if (silent) {
-#pragma unroll
-          for (int q = 0; q < P_UPT; q++) outv[q] = hcur[q];
-        } else {
-          float zi[P_UPT], ri[P_UPT], ni[P_UPT], zr[P_UPT], rr[P_UPT], nr[P_UPT];
-#pragma unroll
-          for (int q = 0; q < P_UPT; q++) {
-            const int u = ub + q;
-            const float h = hcur[q];
-            const float4 pz = *(const float4 *)&prm[16 * u], pr = *(const float4 *)&prm[16 * u + 4];
-            const float4 pn = *(const float4 *)&prm[16 * u + 8], pd = *(const float4 *)&prm[16 * u + 12];
-            zi[q] = (float)az[q] * pz.x + pz.y;
-            ri[q] = (float)ar[q] * pr.x + pr.y;
-            ni[q] = (float)an[q] * pn.x + pn.y;
-            zr[q] = fmaf(pd.x, h, (float)bz[q] * pz.z + pz.w);
-            rr[q] = fmaf(pd.y, h, (float)br[q] * pr.z + pr.w);
-            nr[q] = fmaf(pd.z, h, (float)bn[q] * pn.z + pn.w);
-          }
-          gru_units<P_UPT>(zi, ri, ni, zr, rr, nr, hcur, outv);
-        }
-      } else {
-        int acc[P_UPT];
-        tmem_ld4(t0, acc);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_tempty(ts));
-#pragma unroll
-        for (int q = 0; q < P_UPT; q++) outv[q] = (float)acc[q] * prm[ub + q] + prm[upc + ub + q];
-          if (fabsf(outv[0]) < ACT_FAST_LIMIT && fabsf(outv[1]) < ACT_FAST_LIMIT && fabsf(outv[2]) < ACT_FAST_LIMIT && fabsf(outv[3]) < ACT_FAST_LIMIT) {
-#pragma unroll
-            for (int q = 0; q < P_UPT; q++) outv[q] = act_tanh_inrange(outv[q]);
-          } else {
-#pragma unroll
-            for (int q = 0; q < P_UPT; q++) outv[q] = act_tanh(outv[q]);
-          }
-      }
-      if (live) {
-        *(float4 *)&out_f32[(size_t)srow * N + jq + ub] = make_float4(outv[0], outv[1], outv[2], outv[3]);
-        *(uint32_t *)&out_u8[(size_t)srow * ldo + jq + ub] = quant4(outv[0], outv[1], outv[2], outv[3]);
-      }
-#pragma unroll
-      for (int q = 0; q < P_UPT; q++) { hcur[q] = hnext[q]; if (TC2_HAHEAD == 2) hnext[q] = hnext2[q]; }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(P_TMEM_COLS) : "memory");
+  const int pair = warp / P_PAIR_WARPS, mh = (warp >> 2) & 1;
+  const int r0 = m0 + 64 * mh + frag_row(warp);
+  bool live[2], silent[2];
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int row = r0 + 8 * h;
+    live[h] = row < S;
+    silent[h] = live[h] ? silence[row] != 0 : true;
+    // the row's upc floats = upc / 32 lines of 128 bytes, shared out over the 8 threads of both pairs that own the row
+    if (TC2_H_L2PF && kGru && live[h])
+      for (int l = 4 * pair + (lane & 3); l * 32 < upc; l += 8)
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(&h_old[(size_t)row * N + jq + l * 32]) : "memory");
+  }
+  if (kGru) {   // the parameter records requested in the prologue: own copies landed, then visible to all MMA warps
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * P_EPI_WARPS) : "memory");
+  }
+  mbar_wait(bar_a, 0);
+  const uint32_t aX = smem_u32(sAx) + mh * TC_HALF_BYTES, aH = smem_u32(sAh) + mh * TC_HALF_BYTES;
+  for (int s = pair; s < nslice; s += 2) {
+    const int st = ring_stage(s, TC2_STAGES), ub = s * P_SLICE;   // ub: first unit of the slice inside this CTA's quarter
+    float hold[2][P_UPT];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {   // old state: in flight while the MMAs run
+      if (kGru && live[h]) frag_load_row(h_old + (size_t)(r0 + 8 * h) * N + jq + ub, hold[h]);
+      else
+#pragma unroll
+        for (int q = 0; q < P_UPT; q++) hold[h][q] = 0.f;
+    }
+    int ai[C::kAcc], ar[C::kAcc];
+#pragma unroll
+    for (int i = 0; i < C::kAcc; i++) ai[i] = ar[i] = 0;
+    mbar_wait(bar_bfull(st), (uint32_t)(ring_use(s, TC2_STAGES) & 1));
+    const uint32_t Bs = smem_u32(sB + st * stage_bytes);
+    wgmma_fence();
+    wgmma_chain(ai, aX, TC_A_ATOM_BYTES, Bs, C::kBAtom, natoms);
+    if (kGru) wgmma_chain(ar, aH, TC_A_ATOM_BYTES, Bs + natoms * C::kBAtom, C::kBAtom, natoms);
+    wgmma_commit();
+    wgmma_wait_all();
+    wgmma_hold(ai); wgmma_hold(ar);
+    // the weight stage has been read: hand it back to the producer
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_bempty(st));
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      float outv[P_UPT];
+      if constexpr (kGru) {
+        if (silent[h]) {
+#pragma unroll
+          for (int q = 0; q < P_UPT; q++) outv[q] = hold[h][q];
+        } else {
+          gru_frag<P_SLICE>(ai, ar, prm + 16 * ub, h, hold[h], outv);
+        }
+      } else {
+        conv_frag(ai, prm + ub, prm + upc + ub, h, outv);
+      }
+      const size_t row = (size_t)(r0 + 8 * h);
+      if (live[h]) frag_store_row(out_f32 + row * N + jq + ub, out_u8 + row * ldo + jq + ub, outv);
+    }
   }
 }

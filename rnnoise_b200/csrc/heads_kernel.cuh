@@ -62,9 +62,8 @@ __global__ void __launch_bounds__(32 * NW + 32) k_heads2(int S, DevModel m, cons
   __syncthreads();
   // producer (warp NW): chunk c -> stage c % H2_STAGES.  gru % 64 == 0, so a chunk never straddles two sources.
   // Everything travels as 16-byte cp.async pieces issued by the 32 lanes (activation rows of 256 B per stream into
-  // the padded rows, the 8 KB weight slab): bulk copies cost ~0.5 us EACH on the SM's copy engine whatever their
-  // size -- with two per chunk (weights + VAD weights) the kernel sat at 1.2 us per chunk, 29 us in all, for a
-  // 10 us chain.  Each lane's cp.async.mbarrier.arrive.noinc fires once its pieces have landed: 32 arrivals per phase.
+  // the padded rows, the 8 KB weight slab) rather than bulk copies, which have a fixed cost each on the SM's copy
+  // engine whatever their size, and two of them per chunk (weights + VAD weights) would dominate the FMA chain.  Each lane's cp.async.mbarrier.arrive.noinc fires once its pieces have landed: 32 arrivals per phase.
   auto produce = [&](int c) {
     const int buf = c % H2_STAGES, c0 = c * H2_KC, src = c0 / gru, off = c0 - src * gru;
     const uint32_t bar = smem_u32(&full[buf]);

@@ -1,6 +1,6 @@
 // net_kernel.cuh -- conv1 -> conv2 -> GRU1 -> GRU2 -> GRU3 of compute_rnn() (reference src/rnn.c:44-60) as ONE persistent
-// tcgen05 kernel over a 4-CTA thread-block cluster per 128-stream tile (the default network path; the per-layer
-// kernels k_tc2<> of gru_tc.cuh run the same arithmetic one layer per launch and are kept as cross-checks).
+// wgmma kernel over a 4-CTA thread-block cluster per 128-stream tile (the default network path for small batches; the
+// per-layer kernels k_tc2<> of gru_tc.cuh run the same arithmetic one layer per launch).
 //
 //   cluster = 4 CTAs = one tile of 128 streams; CTA r of the cluster owns output units [r*N/4, (r+1)*N/4) of
 //   EVERY layer.  Per layer a CTA needs the whole u8 activation rows of the previous layer (K = N bytes per
@@ -8,8 +8,8 @@
 //   synchronises (barrier.cluster release/acquire + proxy fence), and every CTA TMA-loads the full 128 x K tile
 //   back from L2.  The recurrent operand Hu8 of the NEXT layer does not depend on this frame, so its TMA load is
 //   issued as soon as the current layer's MMAs have retired and hides behind the epilogue tail; the weight-slice
-//   ring (3 stages) and the TMEM accumulator ring (2 stages) simply run on across layer boundaries, so the weights
-//   of the next layer's first slices are already in shared memory when its activations arrive.
+//   ring (one stage per warpgroup pair) simply runs on across layer boundaries, so the weights of the next layer's first slices are
+//   already in shared memory when its activations arrive.
 //
 //   conv1 (fp32, 195 -> cond, one sequential FMA chain per output: nnet.c:113-123, sgemv vec_avx.h:672) runs as a
 //   prologue on the epilogue warps while the producer prefetches weights: CTA r computes it for streams
@@ -17,10 +17,11 @@
 //   conv1 memory and conv2's u8 operand rows in global memory, and the cluster barrier that starts conv2 publishes
 //   them.  (k_conv1 of rnn_kernels.cuh is the stand-alone cross-check.)
 //
-//   warp 16 (one elected thread): TMA producer + tcgen05.mma issuer      (as in k_tc2)
-//   warps 0..15                 : epilogue, warp w -> TMEM lane quarter w & 3, units 4 * (w >> 2) .. + 4 of a slice
+//   warp 16 (one elected thread)  : TMA producer                                          (as in k_tc2)
+//   warps 0..15 = four warpgroups : MMAs + epilogue; the slices of all layers are numbered in one sequence (jobs) and
+//                                   warpgroup g takes rows 64 (g & 1) .. + 64 of the jobs j with j % 2 == g >> 1
 //
-// Against one launch per layer this removes four kernel boundaries (drain, launch latency, barrier/TMEM/parameter
+// Against one launch per layer this removes four kernel boundaries (drain, launch latency, barrier/parameter
 // prologue, cold TMA pipeline) per frame and lane.  Arithmetic: identical to k_tc2 / the dp4a kernels, bit for bit
 // (exact s32 accumulators; (float)acc*scale + subias; fma(diag,h,.); Pade sigmoid/tanh; h' = z*h + (1-z)*n).
 // grid = (ceil(S/128), R), cluster (1,R,1) with R = 4 or 8, block = 544, dynamic smem = net_smem_bytes(), 1 CTA / SM.
@@ -79,22 +80,15 @@ k_net(int S, int Kc, int Kn, int N, const __grid_constant__ NetMaps maps, const 
   const int stage_bytes = net_stage_bytes(Kn);
   float *prm = (float *)(sB + P_STAGES * stage_bytes);   // conv: [2][upc]; then per GRU layer [upc][16]
   uint64_t *bars = (uint64_t *)(prm + net_prm_floats(N));
-  uint32_t *tmem_slot = (uint32_t *)(bars + 24);
   const uint32_t bar_x = smem_u32(&bars[0]), bar_h = smem_u32(&bars[1]), bar_adone = smem_u32(&bars[2]);
   auto bar_bfull = [&](int i) { return smem_u32(&bars[4 + i]); };
   auto bar_bempty = [&](int i) { return smem_u32(&bars[8 + i]); };
-  auto bar_tfull = [&](int i) { return smem_u32(&bars[12 + i]); };
-  auto bar_tempty = [&](int i) { return smem_u32(&bars[14 + i]); };
 
   if (tid == 0) {
-    mbar_init(bar_x, 1); mbar_init(bar_h, 1); mbar_init(bar_adone, 1);
-    for (int i = 0; i < P_STAGES; i++) { mbar_init(bar_bfull(i), 1); mbar_init(bar_bempty(i), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(bar_tfull(i), 1); mbar_init(bar_tempty(i), P_EPI_WARPS); }
+    // bar_adone: every MMA warp has finished reading the activation tiles of the current layer
+    mbar_init(bar_x, 1); mbar_init(bar_h, 1); mbar_init(bar_adone, P_EPI_WARPS);
+    for (int i = 0; i < P_STAGES; i++) { mbar_init(bar_bfull(i), 1); mbar_init(bar_bempty(i), P_PAIR_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   // epilogue parameters of this CTA's unit quarter, all layers
   for (int i = tid; i < 2 * upc; i += blockDim.x) prm[i] = (i < upc ? p.scale_i[0] : p.subias_i[0])[jq + i % upc];
@@ -106,10 +100,7 @@ k_net(int S, int Kc, int Kn, int N, const __grid_constant__ NetMaps maps, const 
     for (int c = tid; c < 4 * upc; c += blockDim.x) cp_async16(pl + 4 * c, src + 4 * c, true);
   }
   asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
 
   if (p.conv1_w && warp < P_EPI_WARPS) {
     // ---- conv1 prologue for streams [m0 + 32 r, + 32), r = this CTA's rank; the X tile region is still free ----
@@ -187,13 +178,13 @@ k_net(int S, int Kc, int Kn, int N, const __grid_constant__ NetMaps maps, const 
     fence_proxy_async();   // the operand rows are read back by TMA after the cluster barrier
   }
 
+  const int njobs = NET_LAYERS * nslice;
   if (warp == P_EPI_WARPS) {
     // ------------------------------------------------------------------------------------------------
-    // producer / MMA issuer: lane 0 works, the whole warp takes part in the cluster barriers
+    // producer: lane 0 works, the whole warp takes part in the cluster barriers
     // ------------------------------------------------------------------------------------------------
-    int job = 0;   // global slice index over all layers: weight stage job % P_STAGES, TMEM stage job & 1
     auto load_B = [&](int j) {
-      const int L = j / nslice, s = j - L * nslice, st = j % P_STAGES;
+      const int L = j / nslice, s = j - L * nslice, st = ring_stage(j, P_STAGES);
       uint8_t *dst = sB + st * stage_bytes;
       if (L == 0) {
         const int batom = P_SLICE * TC_KATOM;
@@ -209,10 +200,10 @@ k_net(int S, int Kc, int Kn, int N, const __grid_constant__ NetMaps maps, const 
         }
       }
     };
-    const int njobs = NET_LAYERS * nslice;
+    int fed = 0;   // jobs whose weights have been requested
     if (lane == 0) {
       // weights and GRU1's recurrent operand (previous frame's state) do not depend on conv1: fetched beside it
-      for (int j = 0; j < P_STAGES && j < njobs; j++) load_B(j);
+      for (; fed < P_STAGES && fed < njobs; fed++) load_B(fed);
       mbar_expect_tx(bar_h, (uint32_t)(atoms_n * TC_A_ATOM_BYTES));
       for (int a = 0; a < atoms_n; a++) tma_load_2d(smem_u32(sAh + a * TC_A_ATOM_BYTES), &maps.h[1], bar_h, a * TC_KATOM, m0);
     }
@@ -225,48 +216,24 @@ k_net(int S, int Kc, int Kn, int N, const __grid_constant__ NetMaps maps, const 
     }
     for (int L = 0; L < NET_LAYERS; L++) {
       if (lane == 0) {
-        const int natoms = L == 0 ? atoms_c : atoms_n, nmat = L == 0 ? 1 : 2;
-        const int kN = L == 0 ? P_SLICE : 3 * P_SLICE, batom = kN * TC_KATOM;
-        const uint32_t idesc = umma_idesc_i8(TC_M, kN);
-        mbar_wait(bar_x, (uint32_t)(L & 1));
-        if (L >= 1) mbar_wait(bar_h, (uint32_t)((L - 1) & 1));
-        for (int s = 0; s < nslice; s++, job++) {
-          const int st = job % P_STAGES, ts = job & 1;
-          mbar_wait(bar_bfull(st), (uint32_t)((job / P_STAGES) & 1));
-          mbar_wait(bar_tempty(ts), (uint32_t)(((job >> 1) & 1) ^ 1));
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint8_t *Bs = sB + st * stage_bytes;
-          for (int g = 0; g < nmat; g++) {
-            const uint8_t *A = g ? sAh : sAx;
-            for (int a = 0; a < natoms; a++) {
-              const uint64_t ad = umma_desc_sw128(smem_u32(A + a * TC_A_ATOM_BYTES));
-              const uint64_t bd = umma_desc_sw128(smem_u32(Bs + (g * natoms + a) * batom));
-#pragma unroll
-              for (int k = 0; k < TC_KATOM / 32; k++)
-                umma_i8(tmem + ts * (6 * P_SLICE) + g * kN, ad + (uint64_t)(k * 32 >> 4), bd + (uint64_t)(k * 32 >> 4), idesc, (a | k) ? 1u : 0u);
-            }
-          }
-          umma_commit(bar_bempty(st));
-          umma_commit(bar_tfull(ts));
-          if (job >= 1 && job - 1 + P_STAGES < njobs) {   // refill the stage the previous job used
-            mbar_wait(bar_bempty((job - 1) % P_STAGES), (uint32_t)(((job - 1) / P_STAGES) & 1));
-            load_B(job - 1 + P_STAGES);
-          }
+        // the ring runs on into the next layer: job j reuses the stage of job j - P_STAGES (same pair, see ring_stage),
+        // which belongs to this layer or an earlier one, so these waits never depend on the cluster barrier below
+        const int until = (L + 1) * nslice + P_STAGES < njobs ? (L + 1) * nslice + P_STAGES : njobs;
+        for (; fed < until; fed++) {
+          mbar_wait(bar_bempty(ring_stage(fed, P_STAGES)), (uint32_t)((ring_use(fed, P_STAGES) - 1) & 1));
+          load_B(fed);
         }
-        if (L + 1 < NET_LAYERS) {
+        if (L + 1 >= 2 && L + 1 < NET_LAYERS) {
           // the activation tiles are reusable once this layer's MMAs have retired: fetch the next layer's recurrent
-          // operand right away (it only depends on the previous frame)
-          umma_commit(bar_adone);
+          // operand right away (it only depends on the previous frame; GRU1's was loaded in the prologue)
           mbar_wait(bar_adone, (uint32_t)(L & 1));
-          if (L + 1 >= 2) {   // (GRU1's was loaded in the prologue: conv2 does not use the tile)
-            mbar_expect_tx(bar_h, (uint32_t)(atoms_n * TC_A_ATOM_BYTES));
-            for (int a = 0; a < atoms_n; a++) tma_load_2d(smem_u32(sAh + a * TC_A_ATOM_BYTES), &maps.h[L + 1], bar_h, a * TC_KATOM, m0);
-          }
+          mbar_expect_tx(bar_h, (uint32_t)(atoms_n * TC_A_ATOM_BYTES));
+          for (int a = 0; a < atoms_n; a++) tma_load_2d(smem_u32(sAh + a * TC_A_ATOM_BYTES), &maps.h[L + 1], bar_h, a * TC_KATOM, m0);
         }
       }
       if (L + 1 < NET_LAYERS) {
         __syncwarp();
-        cluster_sync_all();   // all four unit quarters of layer L are in global memory
+        cluster_sync_all();   // all unit shares of layer L are in global memory
         if (lane == 0) {
           fence_proxy_async();
           mbar_expect_tx(bar_x, (uint32_t)(atoms_n * TC_A_ATOM_BYTES));
@@ -276,104 +243,92 @@ k_net(int S, int Kc, int Kn, int N, const __grid_constant__ NetMaps maps, const 
     }
   } else {
     // ------------------------------------------------------------------------------------------------
-    // epilogue warps
+    // MMA + epilogue warpgroups
     // ------------------------------------------------------------------------------------------------
     cluster_sync_all();   // (pairs with the producer warp's: conv1 of the whole tile is published)
-    const int lq = warp & 3, ch = warp >> 2;
-    const int srow = m0 + lq * 32 + lane;
-    const bool live = srow < S;
-    const bool silent = live ? silence[srow] != 0 : true;
-    const uint32_t trow = tmem + ((uint32_t)(lq * 32) << 16);
-    int job = 0;
+    const int pair = warp / P_PAIR_WARPS, mh = (warp >> 2) & 1;
+    const int r0 = m0 + 64 * mh + frag_row(warp);
+    bool live[2], silent[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      live[h] = r0 + 8 * h < S;
+      silent[h] = live[h] ? silence[r0 + 8 * h] != 0 : true;
+    }
+    const uint32_t aX = smem_u32(sAx) + mh * TC_HALF_BYTES, aH = smem_u32(sAh) + mh * TC_HALF_BYTES;
     for (int L = 0; L < NET_LAYERS; L++) {
       const float *h_old = p.h_old[L];
       float *out_f32 = p.out_f32[L];
       uint8_t *out_u8 = p.out_u8[L];
       const float *pl = prm + (L == 0 ? 0 : 2 * upc + (L - 1) * 16 * upc);
-      float hcur[P_UPT], hnext[P_UPT];
-      auto load_h = [&](int s, float (&dst)[P_UPT]) {
-        if (L > 0 && live && s < nslice) {
-          float4 a = __ldg((const float4 *)&h_old[(size_t)srow * N + jq + s * P_SLICE + ch * P_UPT]);
-          dst[0] = a.x; dst[1] = a.y; dst[2] = a.z; dst[3] = a.w;
-        } else {
-#pragma unroll
-          for (int q = 0; q < P_UPT; q++) dst[q] = 0.f;
-        }
-      };
-      load_h(0, hcur);
-      for (int s = 0; s < nslice; s++, job++) {
-        const int ts = job & 1;
-        load_h(s + 1, hnext);
-        mbar_wait(bar_tfull(ts), (uint32_t)((job >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t t0 = trow + ts * (6 * P_SLICE) + ch * P_UPT;
-        const int ub = s * P_SLICE + ch * P_UPT;     // unit index inside this CTA's quarter
-        float outv[P_UPT];
+      const int natoms = L == 0 ? atoms_c : atoms_n;
+      mbar_wait(bar_x, (uint32_t)(L & 1));
+      if (L >= 1) mbar_wait(bar_h, (uint32_t)((L - 1) & 1));
+      const int j0 = L * nslice;
+      for (int j = j0 + ((pair - j0) & 1); j < j0 + nslice; j += 2) {
+        const int st = ring_stage(j, P_STAGES), ub = (j - j0) * P_SLICE;   // ub: first unit of the slice inside this CTA's share
+        const uint32_t Bs = smem_u32(sB + st * stage_bytes);
+        float outv[2][P_UPT];
         if (L > 0) {
-          int az[P_UPT], ar[P_UPT], an[P_UPT], bz[P_UPT], br[P_UPT], bn[P_UPT];
-          tmem_ld4(t0 + 0 * P_SLICE, az); tmem_ld4(t0 + 1 * P_SLICE, ar); tmem_ld4(t0 + 2 * P_SLICE, an);
-          tmem_ld4(t0 + 3 * P_SLICE, bz); tmem_ld4(t0 + 4 * P_SLICE, br); tmem_ld4(t0 + 5 * P_SLICE, bn);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+          float hold[2][P_UPT];
+#pragma unroll
+          for (int h = 0; h < 2; h++) {   // old state: in flight while the MMAs run
+            if (live[h]) frag_load_row(h_old + (size_t)(r0 + 8 * h) * N + jq + ub, hold[h]);
+            else
+#pragma unroll
+              for (int q = 0; q < P_UPT; q++) hold[h][q] = 0.f;
+          }
+          int ai[3 * P_SLICE / 2], ar[3 * P_SLICE / 2];
+#pragma unroll
+          for (int i = 0; i < 3 * P_SLICE / 2; i++) ai[i] = ar[i] = 0;
+          mbar_wait(bar_bfull(st), (uint32_t)(ring_use(j, P_STAGES) & 1));
+          wgmma_fence();
+          wgmma_chain_rt(ai, aX, TC_A_ATOM_BYTES, Bs, 3 * P_SLICE * TC_KATOM, natoms);
+          wgmma_chain_rt(ar, aH, TC_A_ATOM_BYTES, Bs + natoms * 3 * P_SLICE * TC_KATOM, 3 * P_SLICE * TC_KATOM, natoms);
+          wgmma_commit();
+          wgmma_wait_all();
+          wgmma_hold(ai); wgmma_hold(ar);
           __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tempty(ts));
-          if (silent) {
+          if (lane == 0) mbar_arrive(bar_bempty(st));
 #pragma unroll
-            for (int q = 0; q < P_UPT; q++) outv[q] = hcur[q];
-          } else {
-            float zi[P_UPT], ri[P_UPT], ni[P_UPT], zr[P_UPT], rr[P_UPT], nr[P_UPT];
+          for (int h = 0; h < 2; h++) {
+            if (silent[h]) {
 #pragma unroll
-            for (int q = 0; q < P_UPT; q++) {
-              const int u = ub + q;
-              const float h = hcur[q];
-              const float4 pz = *(const float4 *)&pl[16 * u], pr = *(const float4 *)&pl[16 * u + 4];
-              const float4 pn = *(const float4 *)&pl[16 * u + 8], pd = *(const float4 *)&pl[16 * u + 12];
-              zi[q] = (float)az[q] * pz.x + pz.y;
-              ri[q] = (float)ar[q] * pr.x + pr.y;
-              ni[q] = (float)an[q] * pn.x + pn.y;
-              zr[q] = fmaf(pd.x, h, (float)bz[q] * pz.z + pz.w);
-              rr[q] = fmaf(pd.y, h, (float)br[q] * pr.z + pr.w);
-              nr[q] = fmaf(pd.z, h, (float)bn[q] * pn.z + pn.w);
+              for (int q = 0; q < P_UPT; q++) outv[h][q] = hold[h][q];
+            } else {
+              gru_frag<P_SLICE>(ai, ar, pl + 16 * ub, h, hold[h], outv[h]);
             }
-            gru_units<P_UPT>(zi, ri, ni, zr, rr, nr, hcur, outv);
           }
         } else {
-          int acc[P_UPT];
-          tmem_ld4(t0, acc);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+          int acc[P_SLICE / 2];
+#pragma unroll
+          for (int i = 0; i < P_SLICE / 2; i++) acc[i] = 0;
+          mbar_wait(bar_bfull(st), (uint32_t)(ring_use(j, P_STAGES) & 1));
+          wgmma_fence();
+          wgmma_chain_rt(acc, aX, TC_A_ATOM_BYTES, Bs, P_SLICE * TC_KATOM, natoms);
+          wgmma_commit();
+          wgmma_wait_all();
+          wgmma_hold(acc);
           __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tempty(ts));
+          if (lane == 0) mbar_arrive(bar_bempty(st));
 #pragma unroll
-          for (int q = 0; q < P_UPT; q++) outv[q] = (float)acc[q] * pl[ub + q] + pl[upc + ub + q];
-          if (fabsf(outv[0]) < ACT_FAST_LIMIT && fabsf(outv[1]) < ACT_FAST_LIMIT && fabsf(outv[2]) < ACT_FAST_LIMIT && fabsf(outv[3]) < ACT_FAST_LIMIT) {
-#pragma unroll
-            for (int q = 0; q < P_UPT; q++) outv[q] = act_tanh_inrange(outv[q]);
-          } else {
-#pragma unroll
-            for (int q = 0; q < P_UPT; q++) outv[q] = act_tanh(outv[q]);
-          }
-        }
-        if (live) {
-          *(float4 *)&out_f32[(size_t)srow * N + jq + ub] = make_float4(outv[0], outv[1], outv[2], outv[3]);
-          *(uint32_t *)&out_u8[(size_t)srow * Kn + jq + ub] = quant4(outv[0], outv[1], outv[2], outv[3]);
+          for (int h = 0; h < 2; h++) conv_frag(acc, pl + ub, pl + upc + ub, h, outv[h]);
         }
 #pragma unroll
-        for (int q = 0; q < P_UPT; q++) hcur[q] = hnext[q];
+        for (int h = 0; h < 2; h++) {
+          const size_t row = (size_t)(r0 + 8 * h);
+          if (live[h]) frag_store_row(out_f32 + row * N + jq + ub, out_u8 + row * Kn + jq + ub, outv[h]);
+        }
       }
       if (L + 1 < NET_LAYERS) {
+        // this warp has finished reading the activation tiles of layer L
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_adone);
         // this thread's part of layer L is written: make it visible to the TMA (async proxy) reads of the whole
         // cluster, then wait until every CTA has done the same
         fence_proxy_async();
         cluster_sync_all();
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(P_TMEM_COLS) : "memory");
   }
   cluster_sync_all();   // no CTA of the cluster exits while a peer could still be arriving on the cluster barrier
 }

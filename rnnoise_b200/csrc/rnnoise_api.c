@@ -43,9 +43,8 @@ struct RNNoiseBatch {
    * each other for good, so every later call fails cleanly instead of producing skewed audio */
   int poisoned;
   /* multi-device batches: one host worker thread per device, so that the enqueue cost of a frame (copies, launches,
-   * event operations: ~60 us of CPU time per device and frame on the host-buffer path) is paid in parallel instead of
-   * G times in a row by the caller's thread -- measured with 8 GPUs from one thread: 0.80 ms per step of enqueueing
-   * against a 0.30 ms GPU step.  A call posts one job per device and returns when all of them are ENQUEUED. */
+   * event operations on the host-buffer path) is paid in parallel instead of G times in a row by the caller's thread,
+   * where it would exceed the GPU step with several devices.  A call posts one job per device and returns when all of them are ENQUEUED. */
   struct Worker *workers;
 };
 

@@ -86,10 +86,12 @@ def test_product_does_not_reference_oracle():
 
 def test_reference_demo_links_unchanged(tmp_path):
     """examples/rnnoise_demo.c of the reference compiles and links against our header + library
-    unmodified (build container only: needs /root/reference)."""
+    unmodified.  Needs the reference sources where oracle/build_ref.py looks for them ($RNNOISE_REFERENCE); skipped
+    where they are absent, because no reference source may be stored in this repository."""
     import subprocess
     import rnnoise_b200
-    demo = "/root/reference/examples/rnnoise_demo.c"
+    from oracle.build_ref import REF
+    demo = os.path.join(REF, "examples", "rnnoise_demo.c")
     if not os.path.exists(demo):
         pytest.skip("reference tree not present")
     exe = str(tmp_path / "rnnoise_demo")

@@ -146,7 +146,7 @@ def test_log_energy_follower_in_float_equals_the_reference_double_form():
 def test_fft_buffer_swizzle_is_a_block_permutation_without_bank_conflicts(emu):
     """dsp_core.cuh `fsw`: a permutation (involution) of every aligned block of 16 complex elements under which every
     FFT stage's half warp (16 lanes x 8-byte elements = one shared-memory wavefront) touches 16 different bank pairs --
-    and the radix-4 m = 4 stage, unswizzled, only 4 (the conflict the swizzle removes, profiles/README.md)."""
+    and the radix-4 m = 4 stage, unswizzled, only 4 (the conflict the swizzle removes)."""
     f = [emu.emu_fsw(i) for i in range(960)]
     assert sorted(f) == list(range(960))
     assert all(f[f[i]] == i and f[i] // 16 == i // 16 for i in range(960))

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Everything goes through the C ABI of
+"""GPU parity tests (run on an H100: pytest -m gpu).  Everything goes through the C ABI of
 include/rnnoise.h (ctypes); the checker is the oracle port (bit-pinned to the reference build by
 tests/test_oracle_port.py) plus the committed reference goldens.
 
@@ -206,7 +206,7 @@ def test_full_size_properties_4096_streams(rb, models_dir):
 
 
 def test_gru_tensor_core_paths_equal_dp4a_path(rb, models_dir):
-    """The tcgen05 GRU kernels (u8 x s8 -> s32 in TMEM; tc2 = persistent pipelined default, tc1 = one tile
+    """The wgmma GRU kernels (u8 x s8 -> s32 in registers; tc2 = persistent pipelined default, tc1 = one tile
     per CTA) and the CUDA-core dp4a kernel accumulate the same exact integers, so whole-pipeline outputs
     and GRU states must be bit-identical; S = 300 exercises a partial 128-row tile (TMA zero fill + guards)."""
     model = rb.Model(os.path.join(models_dir, "hot.bin"))

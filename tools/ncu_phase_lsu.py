@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
 """Shared-memory wavefronts, instructions and sample share per barrier-separated phase of one kernel of an ncu report:
-  python tools/ncu_phase_lsu.py report.ncu-rep NTH_LAUNCH [SMS=148]
+  python tools/ncu_phase_lsu.py report.ncu-rep NTH_LAUNCH [SMS=132]
 (wavefronts / SMS vs share-of-lifetime x cycles tells which phases are bound by the LSU, which by issue slots)."""
 import csv, io, subprocess, sys
 rep, kid = sys.argv[1], sys.argv[2]
-sms = int(sys.argv[3]) if len(sys.argv) > 3 else 148
+sms = int(sys.argv[3]) if len(sys.argv) > 3 else 132   # H100 SXM
 out = subprocess.run(["ncu", "-i", rep, "--page", "source", "--csv", "--kernel-id", ":::" + kid], capture_output=True, text=True).stdout
 lines = out.splitlines()
 print(lines[0][:120])
